@@ -7,13 +7,13 @@ FP32[3,224,224] input (602,112 B) per request, 1000 x FP32 output (4,000 B), con
 load-generation instance per GPU.  A *step* = one closed-loop round of the 64 slots = 64 completed
 requests against the stand-in server (client_b200.testing.native_server: its own process per GPU,
 opens the client's CUDA-IPC handles, runs the model as one batched kernel).  Client and server
-share the GPU through a private CUDA MPS daemon when the box has one (stated in `config.mps`).
+are separate CUDA contexts that time-slice the GPU.
 
   value     the native generator (include/tb200_loadgen.h, `python -m client_b200.perf.loopback`):
             every request's input regenerated on the device inside its IPC region (Philox4x32-10 ->
-            FP32), every response validated on the device; K timed steps (count window), repeated
-            to >= 0.1 s, median repetition; all ranks start together, value = sum of requests /
-            max time.
+            FP32), every response validated on the device; LOOPBACK_REPS timed repetitions of exactly
+            K (--steps) steps each (count windows), median repetition; all ranks start together,
+            value = sum of requests / max time.
   e2e       the same metric through the tritonclient-compatible API, P free-running processes each a
             blocking client (client_b200/perf/host_loop.py): InferenceServerClient.infer ->
             check_shared_memory_region (validated on the device, verdict D2H) +
@@ -27,10 +27,18 @@ share the GPU through a private CUDA MPS daemon when the box has one (stated in 
             perf_analyzer itself does, SURVEY.md section 10).
   roofline  the fill kernel (the dominant kernel of a step): 38,535,168 algorithmic bytes per launch /
             CUDA-event time of back-to-back launches over rotating region sets (> L2), against
-            MEASURED_PEAKS.json hbm_gbs.
+            MEASURED_PEAKS.json hbm_gbs when present, else the H100 SXM data sheet's 3.35 TB/s.
   generator_capacity   the device side of a step alone (fill || validate as graph replays, no server).
   cpu_baseline  the C oracle (oracle/tb200_oracle.c) doing the per-request generation + body marshal
             on one host core.
+
+--dump-outputs DIR writes, after the timed loops, what the in-process device paths computed in their
+last step: generator_capacity and the api loops (generated input tensors, validation results), the
+pack / resize / C3 kernels, the deflate sizes; as DIR/<name>.npy, float32 or float64, large tensors
+as a fixed, seeded sample of DUMP_SAMPLE elements.  Inputs are seeded, so two builds run with the
+same arguments can be compared output for output.  The loopback generator behind `value` runs the
+same fill and validate kernels but is not dumped: which slot it regenerates when depends on when
+responses return, so its tensors differ from run to run.
 
 Multi-GPU: replicas only (SURVEY.md 8e) -- one server + one generator per GPU, each pinned to its
 GPU's share of the local NUMA node's cores (client_b200/perf/topology.py); torch.distributed carries
@@ -61,25 +69,11 @@ SEED = 20260921
 WORKLOAD = "C2 densenet_onnx FP32[3,224,224] --shared-memory=cuda concurrency=64"
 
 
-def profiled_traffic(label):
-    """dram read + write bytes per launch of a kernel from the committed ncu summary
-    (profiles/r0N_<label>_full.txt, written by scripts/summarize_profiles.py; newest round first);
-    the first kernel block of the file.  None if absent."""
-    unit = {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    for tag in ("r02", "r01"):
-        path = os.path.join(ROOT, "profiles", "%s_%s_full.txt" % (tag, label))
-        try:
-            total, seen = 0.0, 0
-            for line in open(path):
-                parts = line.split()
-                if len(parts) == 3 and parts[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum") and seen < 2:
-                    total += float(parts[1].replace(",", "")) * unit.get(parts[2], 1)
-                    seen += 1
-            if seen == 2:
-                return int(total)
-        except OSError:
-            continue
-    return None
+DUMP_SAMPLE = 1 << 20  # elements kept of a larger output by --dump-outputs
+# Timed repetitions of the loopback measurements: two CUDA contexts time-slicing one GPU make a single
+# count window of a few hundred ms swing by tens of per cent from run to run; the median of five does not.
+LOOPBACK_REPS = 5
+GENERATOR_FLOOR_RATE = 1000.0  # requests/s below which a loopback child counts as hung (c=1 runs near 1.7 k on an H100)
 
 
 def measured_peak():
@@ -87,7 +81,25 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
+
+
+def dump_sample(a):
+    """`a` flattened, or a fixed, seeded sample of DUMP_SAMPLE of its elements (in index order)."""
+    flat = np.ascontiguousarray(a).reshape(-1)
+    if flat.size <= DUMP_SAMPLE:
+        return flat
+    idx = np.random.default_rng(SEED).choice(flat.size, DUMP_SAMPLE, replace=False)
+    idx.sort()
+    return flat[idx]
+
+
+def results_for_dump(res):
+    """check results as float64 columns: mismatches, sum (low / high 32 bits), xor32, argmax, max_value"""
+    s = res["sum"].astype(np.uint64)
+    return np.stack([res["mismatches"].astype(np.float64), (s & np.uint64(0xFFFFFFFF)).astype(np.float64),
+                     (s >> np.uint64(32)).astype(np.float64), res["xor32"].astype(np.float64),
+                     res["argmax"].astype(np.float64), res["max_value"].astype(np.float64)], axis=1)
 
 
 class ClockSampler:
@@ -146,6 +158,11 @@ def run_b200(args):
     ctx = _native.Context(local)
     ops = DeviceOps(ctx)
     steps, warmup = args.steps, max(args.warmup, 3)
+    dump = {}  # --dump-outputs: name -> array, taken after each timed loop
+
+    def snapshot_region(name, region, dtype=np.float32):
+        if args.dump_outputs:
+            dump[name] = dump_sample(ops.download(region._base_addr, SLOTS * IN_BYTES).view(dtype).astype(np.float32))
 
     # --- regions: per set one input region (64 slots back to back) and one output region
     in_regions = [cudashm.create_shared_memory_region("bench_in_%d" % s, SLOTS * IN_BYTES, local) for s in range(SETS)]
@@ -192,8 +209,8 @@ def run_b200(args):
     run_steps(max(warmup, GRAPH_STEPS))
     ops.sync()
     rep.barrier()
-    # generator capacity (no server): whole graphs only, at least ~100 ms of device time
-    cap_steps = max(GRAPH_STEPS, (max(steps, 8000) // GRAPH_STEPS) * GRAPH_STEPS)
+    # generator capacity (no server): `steps` steps, graphs of GRAPH_STEPS then single steps
+    cap_steps = steps
     timer.start()
     run_steps(cap_steps)
     timer.stop()
@@ -202,6 +219,10 @@ def run_b200(args):
     ms_cap = rep.max(timer.elapsed_ms())
     res = results_array(results, SETS * SLOTS)
     assert int(res["mismatches"].sum()) == 0, "non-finite logits reported by the validate kernel"
+    last = ((cap_steps % GRAPH_STEPS or GRAPH_STEPS) - 1) % SETS  # the set of the last step run_steps ran
+    snapshot_region("capacity_inputs", in_regions[last])
+    if args.dump_outputs:
+        dump["capacity_results"] = results_for_dump(res[last * SLOTS:(last + 1) * SLOTS])
     cap_value = world * SLOTS * cap_steps / (ms_cap / 1e3)
 
     # --- roofline of the dominant kernel: fill launches only, back to back inside one graph
@@ -241,7 +262,7 @@ def run_b200(args):
     if os.environ.get("TB200_STEP_PARALLEL_MIN_MB"):  # experiment knob (see include/tb200.h)
         _native.check(_native.load().tb200_tune(b"step_parallel_min_mb", int(os.environ["TB200_STEP_PARALLEL_MIN_MB"])))
     # --- e2e: the same step through the public API, job tables H2D + results D2H every step
-    e2e_steps = max(10, min(steps, 20000))
+    e2e_steps = steps
     for i in range(warmup):
         ops.fill(fill_jobs[i % SETS], seed=SEED, epoch=i * SLOTS)
         ops.check(check_jobs[i % SETS], results.device_ptr + (i % SETS) * SLOTS * 32)
@@ -251,7 +272,7 @@ def run_b200(args):
     t0 = time.perf_counter()
     timer.start()
     bad = 0
-    sync_steps = max(10, e2e_steps // 4)
+    sync_steps = steps
     for i in range(sync_steps):
         s = i % SETS
         ops.step(fill_jobs[s], check_jobs[s], results.device_ptr + s * SLOTS * 32, seed=SEED, epoch=i * SLOTS)
@@ -287,12 +308,16 @@ def run_b200(args):
     e2e_ms = rep.max(max(timer.elapsed_ms(), e2e_wall_ms))
     assert bad == 0
     assert SETS > E2E_DEPTH  # steps in flight use different slot sets and result entries
+    last = (e2e_steps - 1) % SETS
+    snapshot_region("api_inputs", in_regions[last])
+    if args.dump_outputs:
+        dump["api_results"] = results_for_dump(res[last * SLOTS:(last + 1) * SLOTS])
     api_value = world * SLOTS * e2e_steps / (e2e_ms / 1e3)
     h2d_step = SLOTS * 64 + (SLOTS + 1) * 4 + SLOTS * 48
     d2h_step = SLOTS * 32
 
     # --- e2e with host tensors: 64 uint8 HWC images (pinned) -> H2D -> cast+scale+CHW pack into the slots
-    img_steps = max(5, min(steps, 2000))
+    img_steps = steps
     images = HostBuffer(SLOTS * 224 * 224 * 3)
     images.array(np.uint8)[:] = np.random.default_rng(1).integers(0, 256, SLOTS * 224 * 224 * 3, dtype=np.uint8)
     staging = DeviceBuffer(local, SLOTS * 224 * 224 * 3)
@@ -328,10 +353,12 @@ def run_b200(args):
     ops.sync()
     pack_ms = timer.elapsed_ms() / (50 * SETS)
     pack_bytes = SLOTS * (224 * 224 * 3) * (1 + 4)
+    snapshot_region("pack_fp32", in_regions[SETS - 1])
     # --- C3 extras (BASELINE configs[2]): one FP16[128,3,224,224] request = 38,535,168 B
     c3_fill = [[make_fill_job(in_regions[s]._base_addr, SLOTS * IN_BYTES, "FP16", stream_id=stream0 + 7000 + s)] for s in range(SETS)]
     # the same chain as the headline roofline: 16,000 back-to-back launches, stream epoch in the parameters
     c3_fill_ms, _ = fill_chain(lambda r, s: ops.fill(c3_fill[s], seed=SEED, epoch=r * SETS + s))
+    snapshot_region("c3_fill_fp16", in_regions[SETS - 1], np.float16)
     c3_src = [DeviceBuffer(local, 128 * 224 * 224 * 3) for _ in range(SETS)]
     ops.fill([make_fill_job(b.ptr, 128 * 224 * 224 * 3, "UINT8", stream_id=stream0 + 7100 + i) for i, b in enumerate(c3_src)], seed=SEED)
     ops.graph_begin()
@@ -348,6 +375,7 @@ def run_b200(args):
     ops.sync()
     c3_pack_ms = timer.elapsed_ms() / (50 * SETS)
     c3_pack_bytes = 128 * 224 * 224 * 3 * (1 + 2)
+    snapshot_region("c3_pack_fp16", in_regions[SETS - 1], np.float16)
     # --- real-image front end: 64 decoded 375x500 RGB photos -> Image.resize(224,224,BILINEAR) ->
     # FP32 CHW INCEPTION, one launch per set (image_client.preprocess after the decode)
     RS_H, RS_W = 375, 500
@@ -367,6 +395,7 @@ def run_b200(args):
     ops.sync()
     rs_ms = timer.elapsed_ms() / (20 * SETS)
     rs_bytes = SLOTS * (RS_H * RS_W * 3 + IN_BYTES)
+    snapshot_region("resize_pack_fp32", in_regions[SETS - 1])
     # --- request-body compression on the device (HTTP Content-Encoding gzip of a generated body)
     import zlib
 
@@ -397,6 +426,8 @@ def run_b200(args):
         dfl.append({"data": label, "in_bytes": dfl_n, "out_bytes": out_bytes, "ratio": round(out_bytes / dfl_n, 4), "ms": round(d_ms, 4),
                     "in_gbps": round(dfl_n / (d_ms / 1e3) / 1e9, 1), "host_zlib6_mbps": round(len(sample) / z_s / 1e6, 1),
                     "host_zlib6_ratio": round(len(zl) / len(sample), 4)})
+    if args.dump_outputs:
+        dump["deflate_out_bytes"] = np.array([d["out_bytes"] for d in dfl], np.float64)
 
     # ------------------------------------------------------------------------------------------
     # the north-star metric: sustained inferences/sec against the stand-in server (one per GPU)
@@ -405,20 +436,17 @@ def run_b200(args):
     nproc, host_cores = host_process_count(world)
     nproc_rank = max(1, nproc // world)
     lb, lb_error = {}, None
-    import shutil
-
-    want_mps = shutil.which("nvidia-cuda-mps-control") is not None and not args.no_mps
     box = None
-    try:  # this rank's GPU: its own MPS daemon, its server
-        box = LoopbackBox([local], use_mps=want_mps, grpc=(world == 1)).__enter__()
+    try:  # this rank's GPU: its server
+        box = LoopbackBox([local], grpc=(world == 1)).__enter__()
     except Exception as ex:
         lb_error = "%s: %s" % (type(ex).__name__, ex)
-    have_mps = rep.sum(1.0 if (box is not None and box.mps) else 0.0) >= world  # every rank got its daemon
     rep.barrier()
-    # every entry takes `sync`, the ranks' rendezvous between "my instance is warm" and "time now"
+    # every entry takes `sync`, the ranks' rendezvous between "my instance is warm" and "time now";
+    # "value" and "once" time exactly LOOPBACK_REPS repetitions of `steps` steps, however long they take
     plan = [("warm", lambda sync: box.generator(local, 50, 5, min_seconds=0.05, sync=sync)),
-            ("value", lambda sync: box.generator(local, steps, warmup, sync=sync)),
-            ("once", lambda sync: box.generator(local, steps, warmup, mode="once", sync=sync)),
+            ("value", lambda sync: box.generator(local, steps, warmup, min_seconds=0, repetitions=LOOPBACK_REPS, sync=sync)),
+            ("once", lambda sync: box.generator(local, steps, warmup, mode="once", min_seconds=0, repetitions=LOOPBACK_REPS, sync=sync)),
             ("warm_host", lambda sync: host_loops(box, "b200", min(nproc_rank, 4), 0.5, "per-request", sync=sync)),
             ("e2e", lambda sync: host_loops(box, "b200", nproc_rank, HOST_LOOP_SECONDS, "device", sync=sync)),
             ("e2e_host", lambda sync: host_loops(box, "b200", nproc_rank, HOST_LOOP_SECONDS, "per-request", sync=sync)),
@@ -446,16 +474,6 @@ def run_b200(args):
     if box is not None:
         box.__exit__(None, None, None)
     rep.barrier()
-    time_sliced = None
-    if world == 1 and have_mps and not args.no_loopback and lb_error is None:
-        try:  # the same run without MPS: client and server are time-sliced CUDA contexts
-            with LoopbackBox([local], use_mps=False) as box:
-                box.generator(local, 50, 5, min_seconds=0.05)
-                g = box.generator(local, min(steps, 2000), warmup, extra=("--device-window-us", "150"), min_seconds=0.5)
-                time_sliced = {"infer_per_s": round(g["infer_per_s"], 1), "p50_us": round(g["p50_us"], 1), "device_window_us": 150,
-                               "slots_per_device_pass": round(g["slots_per_device_pass"], 1)}
-        except Exception as ex:
-            time_sliced = {"error": "%s: %s" % (type(ex).__name__, ex)}
     clocks = sampler.stop()
 
     any_error = rep.sum(0.0 if lb_error is None else 1.0) > 0
@@ -485,7 +503,7 @@ def run_b200(args):
         "n_gpus": world, "steps": steps, "warmup": warmup,
         "ms_per_step": round(ms_step, 6) if ms_step else None, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "u32", "data": "synthetic",
-        "config": common_config(have_mps, world),
+        "config": common_config(world),
         "what": "sustained inferences/sec of the native generator against the stand-in server: every request's FP32[3,224,224] input regenerated "
                 "on the device inside its CUDA-IPC region, every response validated on the device; %d timed steps of %d requests per repetition, "
                 "median of %s repetitions" % (steps, SLOTS, v.get("repetitions")),
@@ -494,7 +512,7 @@ def run_b200(args):
         "slots_per_device_pass": round(v.get("slots_per_device_pass", 0.0), 1), "pipeline_depth": v.get("pipeline_depth"),
         "pinned_cpus_per_generator": v.get("cpus"), "host_cores": host_cores,
         "input_pack_gbps": round(value * IN_BYTES / 1e9, 1),
-        "l2": "inputs of the kernel timings rotate over %d region sets = %d MB > 126 MB L2" % (SETS, SETS * SLOTS * IN_BYTES // 1000000),
+        "l2": "inputs of the kernel timings rotate over %d region sets = %d MB > the 50 MB L2 of an H100" % (SETS, SETS * SLOTS * IN_BYTES // 1000000),
         "e2e": {"value": round(e2e_value, 1), "unit": "infer/s", "h2d_bytes_per_step": SLOTS * (FILL_JOB_BYTES + CHECK_JOB_BYTES), "d2h_bytes_per_step": SLOTS * CHECK_RESULT_BYTES,
                 "processes": nproc_rank * world, "failed_clients": int(total("e2e", "failed_workers")) if lb_error is None else None,
                 "seconds": HOST_LOOP_SECONDS, "p50_us": lb.get("e2e", {}).get("p50_us"),
@@ -511,10 +529,8 @@ def run_b200(args):
         "fill_once": {"value": round(once_value, 1), "e2e": round(e2e_once_value, 1), "p50_us": lb.get("once", {}).get("p50_us"),
                       "what": "regions filled once, every request only names them (perf_analyzer's own behaviour): native generator / drop-in API loop"},
         "gpu_launches": gpu_launches,
-        "roofline": {"bound": "issue (FMA-heavy pipe: 18 IMAD.WIDE per 16 B), then HBM write", "kernel": "fill_uniform_kernel (Philox4x32-10 -> FP32, 64 slots per launch)",
+        "roofline": {"kernel": "fill_uniform_kernel (Philox4x32-10 -> FP32, 64 slots per launch)",
                      "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 4),
-                     "traffic": profiled_traffic("fill_uniform_kernel"),
-                     "traffic_note": "dram__bytes_read.sum + dram__bytes_write.sum per launch of a steady-state launch (rotating sets, no cache control), profiles/r02_fill_uniform_kernel_full.txt",
                      "algorithmic_bytes_per_launch": fill_bytes, "ms_per_launch": round(fill_ms, 6),
                      "peak_source": peak_src, "timing": "CUDA events on the launching stream around %d back-to-back launches (graph replays of 16, stream epoch in the kernel parameters -- the launch a device pass issues)" % fill_launches,
                      "device_epoch_graph": {"ms_per_launch": round(fill_dev_ms, 6), "frac": round(fill_bytes / (fill_dev_ms / 1e3) / 1e9 / peak, 4)},
@@ -531,7 +547,6 @@ def run_b200(args):
         "roofline_pack": {"bound": "hbm", "kernel": "pack_image_chw_tma_kernel (uint8 HWC -> FP32 CHW, INCEPTION)",
                           "achieved": round(pack_bytes / (pack_ms / 1e3) / 1e9, 1), "peak": peak, "unit": "GB/s",
                           "frac": round(pack_bytes / (pack_ms / 1e3) / 1e9 / peak, 4),
-                          "traffic": profiled_traffic("pack_image_kernel"),
                           "algorithmic_bytes_per_launch": pack_bytes, "ms_per_launch": round(pack_ms, 6)},
         "resize_pack": {"kernel": "resize_pack_kernel (64 x uint8 375x500x3 -> Pillow BILINEAR 224x224 -> FP32 CHW INCEPTION)",
                         "ms_per_launch": round(rs_ms, 6), "images_per_s": round(SLOTS / (rs_ms / 1e3), 1),
@@ -550,8 +565,6 @@ def run_b200(args):
         line["loopback_error"] = lb_error
     if "levels" in lb:
         line["loopback_levels"] = lb["levels"]
-    if time_sliced is not None:
-        line["time_sliced_no_mps"] = time_sliced
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         line["cpu_baseline"] = cpu_baseline_port()
     if rank == 0 and world == 1:
@@ -559,6 +572,10 @@ def run_b200(args):
             line["wire_c4_c5"] = wire_extra(ops, ctx, local)
         except Exception as ex:
             line["wire_c4_c5"] = {"error": "%s: %s" % (type(ex).__name__, ex)}
+    if rank == 0 and args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
     if rank == 0:
         print(json.dumps(line), flush=True)
     rep.close()
@@ -641,64 +658,22 @@ def wire_extra(ops, ctx, device, seconds=1.0):
 SERVER_DESC = "client_b200.testing.native_server (own process per GPU, opens the CUDA-IPC handles, batched model kernel)"
 
 
-def common_config(mps, world):
+def common_config(world):
     """The config block both arms print (identical keys and values for the same box)."""
     return {"workload": WORKLOAD, "concurrency": SLOTS, "request_input_bytes": IN_BYTES, "request_output_bytes": OUT_BYTES,
-            "server": SERVER_DESC, "mps": bool(mps), "instances": world}
+            "server": SERVER_DESC, "instances": world}
 
 
 class LoopbackBox:
-    """The serving side of a loopback run: per device one private CUDA MPS daemon (when the box has the binary)
-    and one native server process, pinned to its GPU's server cores.
+    """The serving side of a loopback run: per device one native server process, pinned to its GPU's
+    server cores.  The processes of GPU d see every GPU and address it as ordinal d (`ordinal[d]`);
+    `envs[d]` is the environment they start with."""
 
-    One daemon PER GPU, each started with CUDA_VISIBLE_DEVICES = that GPU: an MPS server takes 48 clients in
-    all, not per device -- one shared daemon on an 8-GPU box refuses most of 8 x (server + generator + API
-    clients) with "device(s) busy or unavailable".  The processes of GPU d therefore run with
-    the daemon's only device, ordinal 0 (`ordinal[d]`; TB200_PIN_GPU names the board index for the CPU pinning,
-    client_b200/perf/topology.physical_index); without MPS they see every GPU and use ordinal d."""
-
-    # per launch (torchrun ranks share MASTER_PORT): a daemon of an earlier run that is still shutting
-    # down cannot be mistaken for ours
-    _TAG = os.environ.get("MASTER_PORT", "") + "_" + str(os.getppid() if os.environ.get("RANK") else os.getpid())
-
-    def __init__(self, devices, use_mps=True, manage_mps=True, grpc=False, pin=True):
-        import shutil
-
+    def __init__(self, devices, grpc=False, pin=True):
         self.devices, self.grpc, self.pin = list(devices), grpc, pin
-        self.mps = self.manage_mps = use_mps and manage_mps and shutil.which("nvidia-cuda-mps-control") is not None
-        self.servers, self.urls, self.grpc_urls, self.envs, self.ordinal = {}, {}, {}, {}, {}
-        self._daemons = []
-        for d in self.devices:
-            self._plain_env(d)
-
-    def _plain_env(self, d):
-        self.envs[d], self.ordinal[d] = dict(os.environ), d
-
-    def _mps_env(self, d):
-        visible = [x.strip() for x in os.environ.get("CUDA_VISIBLE_DEVICES", "").split(",") if x.strip()]
-        phys = visible[d] if d < len(visible) else str(d)
-        tag = "%s_g%d" % (self._TAG, d)
-        board = phys if phys.isdigit() else str(d)  # UUID entries: the position in the list is the best guess for the pinning
-        return dict(os.environ, CUDA_VISIBLE_DEVICES=phys, TB200_PIN_GPU=board, CUDA_MPS_PIPE_DIRECTORY="/tmp/tb200_mps_pipe_" + tag,
-                    CUDA_MPS_LOG_DIRECTORY="/tmp/tb200_mps_log_" + tag)
-
-    def _start_mps(self, d):
-        env = self._mps_env(d)
-        for key in ("CUDA_MPS_PIPE_DIRECTORY", "CUDA_MPS_LOG_DIRECTORY"):
-            os.makedirs(env[key], exist_ok=True)
-        subprocess.run(["nvidia-cuda-mps-control", "-d"], env=env, timeout=30, check=True, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-        self._daemons.append(env)
-        # a client's CUDA_VISIBLE_DEVICES counts in the devices its MPS daemon exposes -- the one GPU, ordinal 0;
-        # which GPU that is on the board (for the CPU pinning) travels in TB200_PIN_GPU
-        self.envs[d], self.ordinal[d] = dict(env, CUDA_VISIBLE_DEVICES="0"), 0
-
-    def _stop_mps(self):
-        for env in self._daemons:
-            try:
-                subprocess.run(["nvidia-cuda-mps-control"], input="quit\n", env=env, text=True, timeout=30, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-            except Exception:
-                pass
-        self._daemons = []
+        self.servers, self.urls, self.grpc_urls = {}, {}, {}
+        self.envs = {d: dict(os.environ) for d in self.devices}
+        self.ordinal = {d: d for d in self.devices}
 
     def _start_server(self, dev):
         import select
@@ -730,24 +705,8 @@ class LoopbackBox:
 
     def __enter__(self):
         try:
-            if self.manage_mps:
-                try:
-                    for d in self.devices:
-                        self._start_mps(d)
-                    time.sleep(1.0)
-                except Exception:  # no daemon to be had: time-sliced contexts
-                    self._stop_mps()
-                    self.mps = self.manage_mps = False
-                    for d in self.devices:
-                        self._plain_env(d)
             for dev in self.devices:
-                try:
-                    self._start_server(dev)
-                except RuntimeError:
-                    if not self.mps:
-                        raise
-                    time.sleep(5.0)  # a daemon of an earlier run may still hold the GPU while it shuts down: once more
-                    self._start_server(dev)
+                self._start_server(dev)
         except Exception:
             self.__exit__(None, None, None)
             raise
@@ -762,18 +721,22 @@ class LoopbackBox:
             except Exception:
                 srv.kill()
         self.servers = {}
-        self._stop_mps()
         return False
 
-    def generator(self, dev, steps, warmup, mode="per-request", concurrency=SLOTS, extra=(), min_seconds=0.1, timeout=120, sync=None):
+    def generator(self, dev, steps, warmup, mode="per-request", concurrency=SLOTS, extra=(), min_seconds=0.1, repetitions=1, sync=None):
         """One `python -m client_b200.perf.loopback` child against this box's server for `dev`.  `sync`: called
         once when the child is warm (or has failed); the child starts timing when it returns -- with one
-        rank per GPU that is the barrier that makes every instance time the same interval."""
+        rank per GPU that is the barrier that makes every instance time the same interval.  min_seconds=0:
+        exactly `repetitions` timed repetitions of `steps` steps.  The child fails by itself when its
+        generator stalls; the time allowed here scales with the requests asked for (start-up + at least
+        GENERATOR_FLOOR_RATE requests/s), so a long run is never cut short."""
         import tempfile
 
+        reps = repetitions if min_seconds <= 0 else 3
+        timeout = 120.0 + (warmup + steps * reps) * concurrency / GENERATOR_FLOOR_RATE + (min_seconds if min_seconds > 0 else 0.0) * 2
         cmd = [sys.executable, "-m", "client_b200.perf.loopback", "-u", self.urls[dev], "--device", str(self.ordinal[dev]), "--concurrency", str(concurrency),
                "--steps", str(steps), "--warmup", str(warmup), "--input-data-mode", mode, "--min-seconds", str(min_seconds),
-               "--seed", str(SEED), "--json"] + (["--pin-cpus"] if self.pin else []) + list(extra)
+               "--repetitions", str(repetitions), "--seed", str(SEED), "--json"] + (["--pin-cpus"] if self.pin else []) + list(extra)
         if sync is None:
             r = subprocess.run(cmd, cwd=ROOT, env=self.envs[dev], capture_output=True, text=True, timeout=timeout)
             stdout, stderr = r.stdout, r.stderr
@@ -825,12 +788,12 @@ def host_loops(box, impl, nproc, seconds, data_mode, sync=None):
     ready, go, q = ctx.Barrier(nproc + 1), ctx.Event(), ctx.Queue()
     devs = box.devices
     procs = []
-    keys = ("CUDA_VISIBLE_DEVICES", "TB200_PIN_GPU", "CUDA_MPS_PIPE_DIRECTORY", "CUDA_MPS_LOG_DIRECTORY")
+    keys = ("CUDA_VISIBLE_DEVICES", "TB200_PIN_GPU")
     saved = {k: os.environ.get(k) for k in keys}
     try:
         for i in range(nproc):
             dev = devs[i % len(devs)]
-            for k in keys:  # a spawned child inherits this process's environment: its GPU's daemon, its GPU as ordinal 0
+            for k in keys:  # a spawned child inherits this process's environment: set its GPU's entries of box.envs
                 if k in box.envs[dev]:
                     os.environ[k] = box.envs[dev][k]
                 else:
@@ -935,7 +898,6 @@ def run_reference(args):
         host_loops(box, "reference", min(nproc, 4), 0.5, "per-request")  # warm-up: contexts, page cache, server
         per_request = host_loops(box, "reference", nproc, HOST_LOOP_SECONDS, "per-request")
         once = host_loops(box, "reference", nproc, HOST_LOOP_SECONDS, "once")
-        mps = box.mps
     value = per_request["infer_per_s"]
     sample = ("%d free-running processes x %.1f s: numpy Generator.random FP32[3,224,224] -> cudaMemcpyAsync H2D + sync (set_shared_memory_region) -> "
               "HTTP infer naming the regions -> whole-region D2H + sync (get_contents_as_numpy); oracle/ref_client.py + oracle/wire.py" % (nproc, HOST_LOOP_SECONDS))
@@ -943,7 +905,7 @@ def run_reference(args):
         "impl": "reference", "metric": "inferences/sec", "value": value, "unit": "infer/s",
         "n_gpus": args.gpus, "steps": steps, "warmup": warmup, "ms_per_step": round(SLOTS / value * 1e3, 4) if value else None,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-        "config": common_config(mps, world),
+        "config": common_config(world),
         "cpu_baseline": {"value": value, "unit": "infer/s", "cores": nproc, "kind": "port", "sample": sample, "host_cores": cores},
         "e2e": {"value": value, "unit": "infer/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "p50_us": per_request["p50_us"], "p99_us": per_request["p99_us"],
@@ -965,8 +927,9 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--no-loopback", action="store_true", help="skip the extra loopback levels (other concurrencies, gRPC configs, the run without MPS)")
-    ap.add_argument("--no-mps", action="store_true", help="do not start a CUDA MPS daemon: client and server time-slice the GPU")
+    ap.add_argument("--no-loopback", action="store_true", help="skip the extra loopback levels (other concurrencies, gRPC configs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed loops write what the device paths computed in their last step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

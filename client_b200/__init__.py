@@ -1,11 +1,11 @@
-"""client_b200 -- a B200-native, tritonclient-compatible client data plane.
+"""client_b200 -- a GPU-native (H100, sm_90a), tritonclient-compatible client data plane.
 
 The package mirrors the module layout of the reference Python client
 (``tritonclient.http``, ``tritonclient.grpc``, ``tritonclient.utils``,
 ``tritonclient.utils.shared_memory``, ``tritonclient.utils.cuda_shared_memory``;
 reference: src/python/library/tritonclient) and adds ``client_b200.perf``, the
 device-side load generator.  Tensor marshalling that the reference does with
-numpy + cudaMemcpy runs as sm_100a CUDA kernels behind the C ABI in
+numpy + cudaMemcpy runs as sm_90a CUDA kernels behind the C ABI in
 ``include/tb200.h`` (``client_b200/lib/libtb200.so``).
 
 ``install_as_tritonclient()`` registers the modules under the ``tritonclient``

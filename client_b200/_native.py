@@ -185,7 +185,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 "libtb200.so not found at %s -- build it with "
-                "`python -m client_b200.build` (nvcc, sm_100a). client_b200 has no "
+                "`python -m client_b200.build` (nvcc, sm_90a). client_b200 has no "
                 "host fallback for its CUDA path." % LIB_PATH
             )
         lib = ctypes.CDLL(LIB_PATH)

@@ -1,4 +1,4 @@
-"""Build libtb200.so (sm_100a) in-tree with nvcc.
+"""Build libtb200.so (sm_90a) in-tree with nvcc.
 
 Used by ``__graft_entry__.build()`` and by developers; the Python modules never
 build implicitly and never fall back to host code when the library is missing.
@@ -16,7 +16,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libtb200.so")
 BUILD = os.path.join(ROOT, "build")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CUFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC"] + ARCH
 SOURCES = ["kernels.cu", "deflate.cu", "runtime.cu", "loadgen.cc", "mock_server.cu"]
 
@@ -36,7 +36,7 @@ def _newer(target, deps):
 
 
 def build_native(force=False, verbose=False):
-    """Compile every CUDA/C++ source for sm_100a and link libtb200.so."""
+    """Compile every CUDA/C++ source for sm_90a and link libtb200.so."""
     os.makedirs(LIBDIR, exist_ok=True)
     os.makedirs(BUILD, exist_ok=True)
     nvcc = _nvcc()

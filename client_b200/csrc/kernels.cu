@@ -1,4 +1,4 @@
-// kernels.cu -- the sm_100a kernels of the tritonclient hot path:
+// kernels.cu -- the sm_90a kernels of the tritonclient hot path:
 //   fill_kernel              synthetic input fill  (Philox4x32-10 -> dtype -> 16 B st.global)
 //   pack_image_chw_tma_kernel uint8 HWC -> fp16/fp32/bf16 CHW, source tiles staged in
 //                            shared memory by TMA bulk copies (cp.async.bulk + mbarrier)
@@ -309,8 +309,7 @@ __global__ void __launch_bounds__(THREADS) fill_unaligned_kernel(const FillLaunc
 // Homogeneous launches (every tensor the same size, dtype and range -- the perf_analyzer
 // case: N slots of one model input): groups of ALL tensors form one index space that the
 // grid walks with a grid stride, so at any moment the chip writes one dense moving window
-// (the access pattern that reaches 6.1-6.8 TB/s in scripts/store_bench.cu, against 5.5 TB/s
-// for one contiguous range per CTA).  Per group only (dst, stream) of its tensor are
+// (scripts/store_bench.cu compares it with one contiguous range per CTA).  Per group only (dst, stream) of its tensor are
 // looked up; the dtype parameters are hoisted out of the loop.
 template <uint32_t DT, int THREADS, int UNROLL, int ROUNDS>
 __global__ void __launch_bounds__(THREADS) fill_stride_kernel(const FillLaunch L) {
@@ -398,8 +397,8 @@ static cudaError_t launch_fill_stride(const FillLaunch& l, uint32_t dtype, int s
 //   * consecutive launches overlap: the kernel releases its dependents at once
 //     (griddepcontrol.launch_dependents) and a successor launched with the programmatic-
 //     serialization attribute starts on the SM slots this grid leaves free, so ramp and tail
-//     of back-to-back fills hide behind each other (6.4 us per 38.5 MB launch in a graph chain
-//     against 7.9 us without; scripts/fill2_bench.cu, profiles/r02_fill2_bench.txt).  Before it
+//     of back-to-back fills hide behind each other (scripts/fill2_bench.cu times a graph chain
+//     with and without; bench.py reports both as roofline.launches_serialised).  Before it
 //     exits every CTA waits for the grid it overlapped with (griddepcontrol.wait), so "this
 //     launch completed" still implies "every earlier launch of the stream completed".
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -447,8 +446,8 @@ constexpr int kFillUniThreads = 256;
 template <uint32_t DT, int CAP, int THREADS, int U, bool PLAIN>
 __global__ void __launch_bounds__(THREADS, 4) fill_uniform_kernel(const __grid_constant__ FillTab<CAP> tab, const __grid_constant__ FillUniform L) {
   // Release the dependents first: the instruction waits for the thread's outstanding loads, and
-  // the epoch load behind it would delay every successor by its latency (7.2 us instead of 6.5 us
-  // per 38.5 MB launch, scripts/fill2_bench.cu modes 3 / 17).  Reading the epoch afterwards is
+  // the epoch load behind it would delay every successor by its latency (scripts/fill2_bench.cu
+  // modes 3 / 17).  Reading the epoch afterwards is
   // safe: the device epoch is only written by a plain kernel behind the chain (the last node of
   // a graph, tb200_graph_end), which starts after the chain's last fill completed, and that
   // implies -- by the griddepcontrol.wait below -- that every fill of the chain completed.
@@ -580,10 +579,10 @@ cudaError_t launch_fill(const FillLaunch& l, int sm_count, cudaStream_t s) {
     if (l.unaligned_jobs == l.njobs && l.bump == 0) return cudaSuccess;  // nothing left for the aligned kernel
   }
   const int v = g_fill_variant;
-  // Default policy (scripts/fill_sweep.py, profiles/): the kernel is issue-bound at 10
-  // Philox rounds, so the cheapest indexing wins: many small equal tensors (wire-mode
-  // slots, a few KB each) take the grid-stride kernel (no per-CTA tensor walk: 2.0 us vs
-  // 4.2 us for 512 x 3 KB), everything else the balanced contiguous ranges.
+  // Default policy (scripts/fill_sweep.py times the alternatives): the kernel is issue-bound
+  // at 10 Philox rounds, so the cheapest indexing wins: many small equal tensors (wire-mode
+  // slots, a few KB each) take the grid-stride kernel (no per-CTA tensor walk), everything
+  // else the balanced contiguous ranges.
   const bool small_homogeneous = l.homogeneous && l.total_groups != 0 && l.uniform_groups * 16 <= 32768;
   if (v == 0) {
     if (small_homogeneous) return launch_fill_stride<256, 4, 10>(l, l.dtype0, sm_count, s, 4);

@@ -1,5 +1,5 @@
 // kernels.cuh -- launch interface between runtime.cu (contexts, regions, ABI)
-// and kernels.cu (the sm_100a kernels).  Internal; the public surface is
+// and kernels.cu (the sm_90a kernels).  Internal; the public surface is
 // include/tb200.h.
 #pragma once
 #include <cuda_runtime.h>

@@ -149,12 +149,12 @@ class CopyPool {
 };
 
 constexpr size_t kStageBytes = 8u << 20;  // one pinned staging buffer
-static size_t kDirectBytes = 2u << 20;    // up to this size the driver's own staging is as fast alone and 1.5x faster when 32 client processes
-                                           // contend (profiles/r02_h2d_compare.txt); "h2d_direct_kb" knob
+static size_t kDirectBytes = 2u << 20;    // up to this size the driver's own staging is used: it holds up better when many client
+                                           // processes contend; "h2d_direct_kb" knob
 constexpr int kStageCount = 4;            // in flight per context
 constexpr size_t kJobSlotBytes = 64u << 10;
 constexpr int kJobSlots = 32;
-constexpr size_t kFlushBytes = 256u << 20;  // > 126 MB L2
+constexpr size_t kFlushBytes = 256u << 20;  // > the 50 MB L2 of an H100
 
 }  // namespace
 

@@ -6,7 +6,7 @@ documented behaviour: keep N requests in flight, synthetic (random / zero) input
 optional system / CUDA shared memory, measurement windows with a stability
 criterion, percentile latency.  Parity with perf_analyzer itself is unpinned.
 
-B200-native part: every concurrency slot owns an input and an output region (CUDA
+GPU-native part: every concurrency slot owns an input and an output region (CUDA
 IPC, registered with the server).  A single device thread serves all slots: the
 slots whose responses came back since the last pass are validated (``check_kernel``)
 and regenerated (``fill_kernel``) with ONE launch each, then handed back to the

@@ -8,14 +8,16 @@ generator, include/tb200_loadgen.h) for ONE GPU, pinned to that GPU's share of t
 A *step* is one closed-loop round of the concurrency slots: ``concurrency`` completed requests.
 After ``warmup`` steps the timed region is exactly ``steps`` steps (a count window,
 tb200_loadgen_wait_count); it is repeated until at least ``--min-seconds`` have been timed and the
-median repetition is reported, so a driver that asks for 20 steps still gets a number that is not
-ramp-up noise.  ``--input-data-mode per-request``: every request's input tensor is regenerated
+median repetition is reported, so a caller that asks for 20 steps still gets a number that is not
+ramp-up noise.  ``--min-seconds 0`` times exactly ``--repetitions`` repetitions of ``steps`` steps,
+however long they take, and reports the median repetition: the work timed depends on the arguments
+alone, and one stall of the host or of the GPU's time slicing moves at most one repetition.
+``--input-data-mode per-request``: every request's input tensor is regenerated
 on the device and every response validated on the device (no tensor byte crosses PCIe); ``once``:
 regions are filled once and requests only name them (what perf_analyzer does, SURVEY.md section 10).
 
-It runs as its own process so that (a) it can be started under CUDA MPS beside the server process
-(two contexts on one GPU otherwise time-slice), (b) its threads can be pinned, (c) a benchmark
-process that already owns a CUDA context does not matter.  bench.py spawns one per GPU.
+It runs as its own process so that (a) its threads can be pinned, (b) a benchmark process that
+already owns a CUDA context does not matter.  bench.py spawns one per GPU.
 """
 
 import argparse
@@ -37,22 +39,42 @@ def rendezvous(sync_dir, timeout=180.0):
         time.sleep(0.001)
 
 
-def measure(gen, concurrency, steps, warmup, min_seconds, max_seconds=20.0, sync_dir=None):
-    """[per-repetition dicts]; a repetition = `steps` x `concurrency` finished requests."""
+def timed_repetition(gen, count, stall_seconds=30.0):
+    """One count window of at least `count` finished requests, however long it takes; raises when the
+    generator finishes nothing for `stall_seconds` (a window is never closed short)."""
+    gen.window(0.0)  # reset: the count window starts here
+    last = -1
+    while True:
+        got = gen.wait_count(count, timeout=stall_seconds)
+        if got >= count:
+            break
+        if got == last:
+            raise RuntimeError("the generator finished no request for %.0f s (%d of %d in the window)" % (stall_seconds, got, count))
+        last = got
+    w = gen.window(0.0)
+    if w["count"] < count:
+        raise RuntimeError("count window closed at %d of %d requests" % (w["count"], count))
+    return w
+
+
+def measure(gen, concurrency, steps, warmup, min_seconds, max_seconds=20.0, sync_dir=None, repetitions=1):
+    """[per-repetition dicts]; a repetition = exactly `steps` x `concurrency` finished requests.
+    min_seconds <= 0: exactly `repetitions` repetitions, whatever their time; otherwise repetitions
+    until `min_seconds` are timed (and 3 repetitions or 1 s), no new one after `max_seconds`."""
     per_rep = steps * concurrency
     gen.window(0.0)
     if warmup > 0:
         gen.wait_count(warmup * concurrency, timeout=30.0)
     if sync_dir:
         rendezvous(sync_dir)
+    if min_seconds <= 0:
+        return [timed_repetition(gen, per_rep) for _ in range(max(1, repetitions))]
     reps, timed, t_start = [], 0.0, time.perf_counter()
     while True:
-        gen.window(0.0)  # reset: the count window starts here
-        gen.wait_count(per_rep, timeout=max(5.0, max_seconds))
-        w = gen.window(0.0)
+        w = timed_repetition(gen, per_rep)
         reps.append(w)
         timed += w["seconds"]
-        if (timed >= min_seconds and len(reps) >= 3) or (timed >= min_seconds and timed >= 1.0) or time.perf_counter() - t_start > max_seconds:
+        if (timed >= min_seconds and (len(reps) >= 3 or timed >= 1.0)) or time.perf_counter() - t_start > max_seconds:
             break
     return reps
 
@@ -66,6 +88,7 @@ def main(argv=None):
     ap.add_argument("--steps", type=int, default=2000)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--min-seconds", type=float, default=0.1)
+    ap.add_argument("--repetitions", type=int, default=1, help="with --min-seconds 0: timed repetitions of --steps steps (median reported)")
     ap.add_argument("--input-data-mode", default="per-request", choices=["per-request", "once"])
     ap.add_argument("--device-pipeline", type=int, default=3)
     ap.add_argument("--device-window-us", type=int, default=0)
@@ -100,7 +123,7 @@ def main(argv=None):
                               pipeline_depth=args.device_pipeline)
     gen.start()
     try:
-        reps = measure(gen, args.concurrency, args.steps, args.warmup, args.min_seconds, sync_dir=args.sync_dir)
+        reps = measure(gen, args.concurrency, args.steps, args.warmup, args.min_seconds, sync_dir=args.sync_dir, repetitions=args.repetitions)
     finally:
         gen.stop()
         ss.unregister(control)

@@ -111,7 +111,7 @@ def physical_index(device_id):
     """The nvidia-smi index behind CUDA ordinal ``device_id``: CUDA_VISIBLE_DEVICES renumbers the devices a
     process sees, sysfs and nvidia-smi do not.  (UUID entries cannot be mapped here and leave the ordinal.)"""
     forced = os.environ.get("TB200_PIN_GPU", "").strip()  # set by whoever remapped the devices in a way this cannot see
-    if forced.isdigit():                                   # (an MPS daemon started on one GPU: its clients see ordinal 0)
+    if forced.isdigit():                                   # (e.g. a container that exposes one board as ordinal 0)
         return int(forced)
     parts = [x.strip() for x in os.environ.get("CUDA_VISIBLE_DEVICES", "").split(",") if x.strip()]
     if parts and all(x.isdigit() for x in parts) and 0 <= int(device_id) < len(parts):

@@ -281,7 +281,7 @@ def destroy_shared_memory_region(cuda_shm_handle):
 
 
 # ---------------------------------------------------------------------------
-# B200-native producers / consumers (no counterpart in the reference: there the
+# GPU-native producers / consumers (no counterpart in the reference: there the
 # data always starts in a numpy array and is copied with cudaMemcpy).
 # ---------------------------------------------------------------------------
 def fill_shared_memory_region(

@@ -1,5 +1,5 @@
 /*
- * tb200.h -- C ABI of libtb200.so, the B200-native data plane behind the
+ * tb200.h -- C ABI of libtb200.so, the GPU-native data plane behind the
  * tritonclient-compatible Python package `client_b200`.
  *
  * Every entry point is plain C: pointers, sizes, opaque handles.  No torch,

@@ -32,9 +32,11 @@ TESTS = ["client_timeout_test", "memory_leak_test"]  # cudaMalloc + cudaIpcGetMe
 
 
 def build_ref_examples(force=False):
-    """Returns {name: path}; {} when the reference tree or g++ is absent."""
+    """Returns {name: path}.  Without the reference tree or g++: the programs built earlier that are
+    still in OUT (they travel with the working tree to machines that have no reference tree)."""
     if not os.path.isdir(REF) or shutil.which("g++") is None:
-        return {}
+        found = {n: os.path.join(OUT, n) for n in EXAMPLES + GRPC_EXAMPLES + CUDA_EXAMPLES + TESTS}
+        return {n: p for n, p in found.items() if os.access(p, os.X_OK)}
     from client_b200.build import build_cpp_client, build_native
 
     build_native()

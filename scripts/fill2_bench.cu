@@ -3,8 +3,8 @@
 // Philox4x32-10 contract of client_b200/csrc/philox.cuh, and the launch mechanics around
 // them (plain stream, programmatic dependent launch, graph chains, two streams).
 //
-//   nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_100a,code=sm_100a -o /tmp/fill2_bench scripts/fill2_bench.cu
-//   /tmp/fill2_bench            (GPU box; prints one line per variant x mechanism)
+//   nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a -o fill2_bench scripts/fill2_bench.cu
+//   ./fill2_bench               (prints one line per variant x mechanism)
 //
 // Every variant is checked bit for bit against a host restatement of the contract before
 // it is timed.
@@ -280,7 +280,8 @@ struct Variant {
   int per_sm;      // target CTAs per SM
 };
 
-static int g_sms = 148;
+static int g_sms = 0;  // set from the device in main
+static double g_peak_gbs = 0;  // the device's theoretical DRAM bandwidth (memory clock x bus width, DDR), set in main
 static uint8_t* g_buf = nullptr;
 static const uint64_t kSlot = 602112, kSet = 64 * kSlot;
 static RK g_rk;
@@ -474,7 +475,11 @@ int main(int argc, char** argv) {
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, dev));
   g_sms = prop.multiProcessorCount;
-  printf("# %s, %d SMs\n", prop.name, g_sms);
+  int mem_khz = 0, bus_bits = 0;
+  CK(cudaDeviceGetAttribute(&mem_khz, cudaDevAttrMemoryClockRate, dev));
+  CK(cudaDeviceGetAttribute(&bus_bits, cudaDevAttrGlobalMemoryBusWidth, dev));
+  g_peak_gbs = 2.0 * mem_khz * 1e3 * (bus_bits / 8) / 1e9;
+  printf("# %s, %d SMs, theoretical DRAM bandwidth %.0f GB/s (frac below is of this)\n", prop.name, g_sms, g_peak_gbs);
   CK(cudaMalloc(&g_buf, 4 * kSet));
   uint32_t k0 = (uint32_t)kSeed, k1 = (uint32_t)(kSeed >> 32);
   for (int r = 0; r < 10; ++r) { g_rk.k[2 * r] = k0; g_rk.k[2 * r + 1] = k1; k0 += W0; k1 += W1; }
@@ -520,7 +525,7 @@ int main(int argc, char** argv) {
       if (!ok) continue;
       for (int m = 0; m < 5; ++m) {
         const double us = time_variant(v, c3, m, launches);
-        if (us > 0) printf("    %-10s %7.2f us  %6.0f GB/s  frac %.3f\n", mech_name[m], us, kSet / us / 1e3, kSet / us / 1e3 / 6574.8);
+        if (us > 0) printf("    %-10s %7.2f us  %6.0f GB/s  frac %.3f\n", mech_name[m], us, kSet / us / 1e3, kSet / us / 1e3 / g_peak_gbs);
       }
       fflush(stdout);
     }

@@ -1,6 +1,6 @@
 """Time the fill kernel variants (tb200_tune fill_variant) on one GPU.
 
-Usage (GPU box):  python scripts/fill_sweep.py > gpurun_out/fill_sweep.txt
+Usage:  python scripts/fill_sweep.py > fill_sweep.txt
 For each variant: FP32 C2 step (64 x 602,112 B), FP16 C3 tensor (38,535,168 B), the C4
 wire shape (512 x 3,072 B INT64) and a 256-slot launch (154 MB), all timed with CUDA
 events around back-to-back launches inside one CUDA graph, rotating over > L2 of memory.

@@ -1,10 +1,12 @@
 // philox_bench.cu -- how fast can an SM run Philox4x32-10?  (experiment aid, not product)
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o /tmp/philox_bench scripts/philox_bench.cu && /tmp/philox_bench
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o philox_bench scripts/philox_bench.cu && ./philox_bench
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>
 
 struct RK { uint32_t k[20]; };
+static int g_sms = 0;        // SMs of the device (main)
+static double g_clock_hz = 0;  // its maximum SM clock
 
 template <int MODE>
 __device__ __forceinline__ void round1(uint32_t& c0, uint32_t& c1, uint32_t& c2, uint32_t& c3, uint32_t k0, uint32_t k1) {
@@ -54,7 +56,7 @@ __global__ void __launch_bounds__(256) k_philox(uint4* out, uint32_t iters, cons
 template <int MODE, int ILP, int STORE>
 void run(const char* name, uint4* buf, int ctas_per_sm, uint32_t iters) {
   RK rk; for (int i = 0; i < 20; ++i) rk.k[i] = 0x9E3779B9u * (i + 1);
-  const int grid = 148 * ctas_per_sm;
+  const int grid = g_sms * ctas_per_sm;
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
   k_philox<MODE, ILP, STORE><<<grid, 256>>>(buf, iters, rk);
   cudaDeviceSynchronize();
@@ -63,13 +65,17 @@ void run(const char* name, uint4* buf, int ctas_per_sm, uint32_t iters) {
   cudaEventRecord(b); cudaEventSynchronize(b);
   float ms; cudaEventElapsedTime(&ms, a, b);
   const double calls = (double)grid * 256 * iters * ILP;        // thread-calls
-  const double warp_calls_per_smsp = calls / 32 / (148 * 4);
-  const double cycles = ms * 1e-3 * 1.965e9;
+  const double warp_calls_per_smsp = calls / 32 / (g_sms * 4.0);
+  const double cycles = ms * 1e-3 * g_clock_hz;
   printf("%-44s ctas/sm=%d  %8.3f ms  %6.1f cycles/warp-call/SMSP  -> %6.0f GB/s of 16 B groups%s\n", name, ctas_per_sm, ms,
          cycles / warp_calls_per_smsp, calls * 16 / (ms * 1e-3) / 1e9, STORE ? " (stored)" : "");
 }
 
 int main() {
+  int clock_khz = 0;
+  cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0);
+  cudaDeviceGetAttribute(&clock_khz, cudaDevAttrClockRate, 0);
+  g_clock_hz = clock_khz * 1e3;
   uint4* buf; cudaMalloc(&buf, (size_t)1 << 30);
   for (int cps : {2, 4, 6, 8}) {
     run<0, 1, 0>("imad.wide ilp1 compute only", buf, cps, 2000);

@@ -1,6 +1,6 @@
 // store_bench.cu -- micro-benchmark of write-only access patterns on one GPU (experiment
 // aid for the fill kernel; not part of the product).  Build+run on the GPU box:
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o /tmp/store_bench scripts/store_bench.cu && /tmp/store_bench
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o store_bench scripts/store_bench.cu && ./store_bench
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>
@@ -77,6 +77,8 @@ template <typename F> float time_it(F launch, cudaStream_t s, int reps, int sets
 }
 
 int main() {
+  int sms = 0;
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
   const uint64_t small = 38535168, total = 4 * small;
   uint4* buf; CK(cudaMalloc(&buf, total));
   cudaStream_t s; CK(cudaStreamCreate(&s));
@@ -87,7 +89,7 @@ int main() {
     printf("== %s\n", c.name);
     float ms = time_it([&](int k) { cudaMemsetAsync((char*)buf + (c.sets > 1 ? k * small : 0), 0, c.bytes, s); }, s, 4, c.sets);
     printf("%-40s %8.2f us %8.0f GB/s\n", "cudaMemsetAsync", ms * 1e3, c.bytes / ms / 1e6);
-    int grids[] = {148 * 2, 148 * 4, 148 * 6, 148 * 8, 148 * 16, 148 * 32};
+    int grids[] = {sms * 2, sms * 4, sms * 6, sms * 8, sms * 16, sms * 32};
     for (int g : grids) {
       char nm[64];
 #define RUN(label, kern) { ms = time_it([&](int k) { kern<<<g, 256, 0, s>>>(buf + (c.sets > 1 ? k * (small / 16) : 0), n, k); }, s, 4, c.sets); \

@@ -1,6 +1,5 @@
-"""Host logic of bench.py that needs no GPU: which MPS daemon / device ordinal / pinning hint the processes
-of GPU d get (an MPS server takes 48 clients in all, so every GPU has its own daemon; clients of a daemon
-started on one GPU address it as ordinal 0), and how the client processes of a box are spawned."""
+"""Host logic of bench.py that needs no GPU: which device ordinal and environment the processes of GPU d
+get, and how the client processes of a box are spawned."""
 
 import os
 import subprocess
@@ -13,50 +12,11 @@ if ROOT not in sys.path:
 import bench  # noqa: E402
 
 
-def test_per_gpu_daemon_environment(monkeypatch):
-    monkeypatch.setattr(bench.shutil if hasattr(bench, "shutil") else __import__("shutil"), "which", lambda name: "/usr/bin/" + name)
-    calls = []
-
-    def fake_run(cmd, **kw):
-        calls.append((cmd, kw.get("env", {}), kw.get("input")))
-        return subprocess.CompletedProcess(cmd, 0)
-
-    monkeypatch.setattr(bench.subprocess, "run", fake_run)
-    monkeypatch.setenv("CUDA_VISIBLE_DEVICES", "4,6")  # the launcher gave this job boards 4 and 6
-    box = bench.LoopbackBox([0, 1])
-    assert box.mps and box.ordinal == {0: 0, 1: 1}  # nothing started yet: plain environment
-    for d in box.devices:
-        box._start_mps(d)
-    # the daemons own one board each ...
-    assert [c[1]["CUDA_VISIBLE_DEVICES"] for c in calls] == ["4", "6"]
-    assert calls[0][1]["CUDA_MPS_PIPE_DIRECTORY"] != calls[1][1]["CUDA_MPS_PIPE_DIRECTORY"]
-    # ... and their clients see it as the daemon's device 0, with the board index for the CPU pinning
-    for d, board in ((0, "4"), (1, "6")):
-        env = box.envs[d]
-        assert env["CUDA_VISIBLE_DEVICES"] == "0" and env["TB200_PIN_GPU"] == board and box.ordinal[d] == 0
-        assert env["CUDA_MPS_PIPE_DIRECTORY"] == calls[d][1]["CUDA_MPS_PIPE_DIRECTORY"]
-    box._stop_mps()
-    quits = [c for c in calls if c[2] == "quit\n"]
-    assert len(quits) == 2 and {q[1]["CUDA_MPS_PIPE_DIRECTORY"] for q in quits} == {c[1]["CUDA_MPS_PIPE_DIRECTORY"] for c in calls[:2]}
-
-
-def test_uuid_device_lists_keep_the_daemon_on_its_gpu(monkeypatch):
-    import shutil
-
-    monkeypatch.setattr(shutil, "which", lambda name: "/usr/bin/" + name)
-    monkeypatch.setenv("CUDA_VISIBLE_DEVICES", "GPU-aaaa,GPU-bbbb")
-    env = bench.LoopbackBox([0, 1])._mps_env(1)
-    assert env["CUDA_VISIBLE_DEVICES"] == "GPU-bbbb" and env["TB200_PIN_GPU"] == "1"
-
-
-def test_without_the_mps_binary_processes_see_every_gpu(monkeypatch):
-    import shutil
-
-    monkeypatch.setattr(shutil, "which", lambda name: None)
+def test_processes_see_every_gpu(monkeypatch):
     monkeypatch.delenv("CUDA_VISIBLE_DEVICES", raising=False)
     box = bench.LoopbackBox([0, 3])
-    assert not box.mps and box.ordinal == {0: 0, 3: 3}
-    assert "CUDA_MPS_PIPE_DIRECTORY" not in box.envs[3] and "TB200_PIN_GPU" not in box.envs[3]
+    assert box.ordinal == {0: 0, 3: 3}
+    assert "CUDA_VISIBLE_DEVICES" not in box.envs[3] and "TB200_PIN_GPU" not in box.envs[3]
 
 
 def _env_probe(impl, url, device, tag, seconds, data_mode, ready, go, q):
@@ -64,33 +24,32 @@ def _env_probe(impl, url, device, tag, seconds, data_mode, ready, go, q):
     import json
 
     with open(os.path.join(url, tag + ".json"), "w") as fh:
-        json.dump([device, os.environ.get("CUDA_VISIBLE_DEVICES"), os.environ.get("TB200_PIN_GPU"), os.environ.get("CUDA_MPS_PIPE_DIRECTORY")], fh)
+        json.dump([device, os.environ.get("CUDA_VISIBLE_DEVICES"), os.environ.get("TB200_PIN_GPU")], fh)
     ready.wait()
     go.wait()
     q.put((1, [1000.0], None))
 
 
 def test_host_loop_children_inherit_their_gpus_environment(monkeypatch, tmp_path):
-    """host_loops spawns the clients of GPU d with d's daemon and ordinal, and leaves this process's environment alone"""
+    """host_loops spawns the clients of GPU d with d's environment and ordinal, and leaves this process's environment alone"""
     import json
 
     class Box:
         devices = [0, 1]
         urls = {0: str(tmp_path), 1: str(tmp_path)}
         ordinal = {0: 0, 1: 0}
-        envs = {0: {"CUDA_VISIBLE_DEVICES": "0", "TB200_PIN_GPU": "4", "CUDA_MPS_PIPE_DIRECTORY": "/tmp/p4"},
-                1: {"CUDA_VISIBLE_DEVICES": "0", "TB200_PIN_GPU": "6", "CUDA_MPS_PIPE_DIRECTORY": "/tmp/p6"}}
+        envs = {0: {"CUDA_VISIBLE_DEVICES": "4", "TB200_PIN_GPU": "4"},
+                1: {"CUDA_VISIBLE_DEVICES": "6", "TB200_PIN_GPU": "6"}}
 
     monkeypatch.setenv("CUDA_VISIBLE_DEVICES", "4,6")
     monkeypatch.delenv("TB200_PIN_GPU", raising=False)
-    monkeypatch.delenv("CUDA_MPS_PIPE_DIRECTORY", raising=False)
     monkeypatch.setattr(bench, "_host_loop_worker", _env_probe)
     synced = []
     out = bench.host_loops(Box, "b200", 4, 0.01, "once", sync=lambda: synced.append(1))
     assert out["count"] == 4 and out["processes"] == 4 and out["failed_workers"] == 0 and synced == [1]
     seen = sorted(tuple(json.load(open(os.path.join(str(tmp_path), f)))) for f in os.listdir(str(tmp_path)))
-    assert seen == sorted([(0, "0", "4", "/tmp/p4"), (0, "0", "6", "/tmp/p6")] * 2)
-    assert os.environ["CUDA_VISIBLE_DEVICES"] == "4,6" and "TB200_PIN_GPU" not in os.environ and "CUDA_MPS_PIPE_DIRECTORY" not in os.environ
+    assert seen == sorted([(0, "4", "4"), (0, "6", "6")] * 2)
+    assert os.environ["CUDA_VISIBLE_DEVICES"] == "4,6" and "TB200_PIN_GPU" not in os.environ
 
 
 FAKE_CHILD = """#!%s
@@ -106,7 +65,7 @@ if sync_dir:
         time.sleep(0.001)
         assert time.time() - t0 < 20
 print(json.dumps({"infer_per_s": 123.0, "device": int(args[args.index("--device") + 1]), "synced": bool(sync_dir),
-                  "pipe": os.environ.get("CUDA_MPS_PIPE_DIRECTORY")}))
+                  "pin": os.environ.get("TB200_PIN_GPU")}))
 """
 
 
@@ -121,12 +80,12 @@ def test_generator_child_is_released_by_the_rendezvous(monkeypatch, tmp_path):
     monkeypatch.setattr(shutil, "which", lambda name: None)
     box = bench.LoopbackBox([2])
     box.urls[2] = "127.0.0.1:9"
-    box.envs[2] = dict(os.environ, CUDA_MPS_PIPE_DIRECTORY="/tmp/pipe_g2")
+    box.envs[2] = dict(os.environ, TB200_PIN_GPU="5")
     box.ordinal[2] = 0
     monkeypatch.setattr(sys, "executable", str(fake))
     order = []
     g = box.generator(2, 20, 5, sync=lambda: order.append("sync"))
-    assert g == {"infer_per_s": 123.0, "device": 0, "synced": True, "pipe": "/tmp/pipe_g2"} and order == ["sync"]
+    assert g == {"infer_per_s": 123.0, "device": 0, "synced": True, "pin": "5"} and order == ["sync"]
     assert box.generator(2, 20, 5)["synced"] is False  # no rendezvous asked for: plain run
     import pytest
 

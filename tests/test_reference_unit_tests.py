@@ -7,6 +7,7 @@ and test_shared_memory.py (SURVEY.md section 4).  Each is loaded with `client_b2
 `tritonclient` and run by unittest in a fresh interpreter."""
 
 import filecmp
+import hashlib
 import os
 import subprocess
 import sys
@@ -31,9 +32,14 @@ def _run(module_file, timeout=300):
 
 @pytest.mark.parametrize("name", ["test_cuda_shared_memory.py", "test_shared_memory.py"])
 def test_fixture_copies_are_the_reference_files(name):
-    if not os.path.isdir(REF):
-        pytest.skip("reference tree not mounted")
-    assert filecmp.cmp(os.path.join(FIX, name), os.path.join(REF, name), shallow=False)
+    """The copies hash to the SHA-256 digests taken from the reference's own files (golden/reference_tests/SHA256SUMS);
+    where the reference tree is mounted they are also compared with it byte for byte."""
+    with open(os.path.join(FIX, "SHA256SUMS")) as fh:
+        want = dict(line.split()[::-1] for line in fh if line.strip())
+    with open(os.path.join(FIX, name), "rb") as fh:
+        assert hashlib.sha256(fh.read()).hexdigest() == want[name]
+    if os.path.isdir(REF):
+        assert filecmp.cmp(os.path.join(FIX, name), os.path.join(REF, name), shallow=False)
 
 
 def test_reference_system_shared_memory_unit_tests_unmodified():

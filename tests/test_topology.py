@@ -6,7 +6,7 @@ from client_b200.perf import topology
 
 
 def _gpus():
-    # the 8-GPU box of SCALE_r01: GPU0-3 -> 0-31,64-95; GPU4-7 -> 32-63,96-127
+    # an 8-GPU box with two NUMA nodes: GPU0-3 -> 0-31,64-95; GPU4-7 -> 32-63,96-127
     a, b = topology.parse_cpulist("0-31,64-95"), topology.parse_cpulist("32-63,96-127")
     return [{"index": i, "bus_id": "x", "numa_node": 0 if i < 4 else 1, "ranges": a if i < 4 else b} for i in range(8)]
 
@@ -62,7 +62,7 @@ def test_physical_index_follows_cuda_visible_devices(monkeypatch):
     assert topology.physical_index(4) == 4  # out of range: left alone
     monkeypatch.setenv("CUDA_VISIBLE_DEVICES", "GPU-8f6c1e2a")
     assert topology.physical_index(0) == 0
-    monkeypatch.setenv("CUDA_VISIBLE_DEVICES", "0")  # a client of an MPS daemon that owns GPU 6
+    monkeypatch.setenv("CUDA_VISIBLE_DEVICES", "0")  # a container that exposes board 6 as its only device
     monkeypatch.setenv("TB200_PIN_GPU", "6")
     assert topology.physical_index(0) == 6
 
