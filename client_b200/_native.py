@@ -158,6 +158,7 @@ SIGNATURES = {
     "tb200_step_sync": (c_int, [c_vp, ctypes.POINTER(FillJob), c_int, c_u64, c_u64, ctypes.POINTER(CheckJob), c_int, c_vp]),
     "tb200_step_submit": (c_int, [c_vp, ctypes.POINTER(FillJob), c_int, c_u64, c_u64, ctypes.POINTER(CheckJob), c_int, c_vp, ctypes.POINTER(c_u64)]),
     "tb200_step_wait": (c_int, [c_vp, c_u64]),
+    "tb200_step_submit_copy": (c_int, [c_vp, ctypes.POINTER(CopyJob), c_int, ctypes.POINTER(CheckJob), c_int, c_vp, ctypes.POINTER(c_u64)]),
 }
 
 _lib = None

@@ -2,7 +2,7 @@
 
 import ctypes
 
-from ._native import CheckJob, FillJob
+from ._native import CheckJob, CopyJob, FillJob
 
 c_vp, c_u64, c_int = ctypes.c_void_p, ctypes.c_uint64, ctypes.c_int
 
@@ -20,6 +20,8 @@ class LoadgenConfig(ctypes.Structure):
         ("device_window_us", ctypes.c_uint32), ("protocol", ctypes.c_uint32), ("grpc_path", ctypes.c_char_p),
         ("lookahead", ctypes.c_uint32), ("tail_stride", c_u64), ("requests_per_slot", ctypes.c_uint32),
         ("pipeline_depth", ctypes.c_uint32),
+        ("replay_entries", c_u64), ("copy_jobs", ctypes.POINTER(CopyJob)), ("copy_jobs_per_slot", c_int),
+        ("copy_src_stride", ctypes.POINTER(c_u64)), ("check_b_stride", ctypes.POINTER(c_u64)),
     ]
 
 
@@ -44,6 +46,7 @@ LOADGEN_SIGNATURES = {
     "tb200_loadgen_wait_count": (c_int, [c_vp, c_u64, ctypes.c_double, ctypes.POINTER(c_u64)]),
     "tb200_loadgen_stop": (c_int, [c_vp]),
     "tb200_loadgen_destroy": (c_int, [c_vp]),
+    "tb200_loadgen_replay_entry": (c_u64, [c_u64, c_u64, ctypes.c_uint32, c_int, c_u64]),
     "tb200_stub_server_start": (c_int, [ctypes.c_char_p, ctypes.POINTER(c_int), ctypes.c_char_p, ctypes.POINTER(c_vp)]),
     "tb200_stub_server_stop": (c_int, [c_vp]),
     "tb200_grpc_stub_server_start": (c_int, [ctypes.c_char_p, ctypes.POINTER(c_int), c_vp, c_u64, ctypes.POINTER(c_vp)]),

@@ -201,11 +201,52 @@ struct tb200_loadgen {
   uint64_t device_batches = 0, device_slots = 0, nonfinite = 0, mismatches = 0, epoch = 0;
   std::string error;
   uint64_t window_start_ns = 0;
+  // replayed inputs (cfg.replay_entries != 0): copy and check templates point at entry 0.  Kept
+  // behind every other member, so the members the transport and device threads share keep the
+  // layout they have in a run without replay.
+  uint64_t replay_entries = 0;
+  std::vector<tb200_copy_job> copy_jobs;
+  int copy_per_slot = 0;
+  std::vector<uint64_t> copy_stride, check_b_stride;
+  std::vector<uint64_t> replay_gen;  // per slot: the generation its inputs hold (device thread only)
 };
 
 namespace {
 
 constexpr uint32_t kEvTag = 0xFFFFFFFFu;
+
+// replayed inputs: the entry image g of slot s's current generation carries
+uint64_t replay_entry_of(const tb200_loadgen* lg, int s, int g) {
+  return tb200_loadgen_replay_entry(static_cast<uint64_t>(s), lg->replay_gen[static_cast<size_t>(s)] * lg->lookahead + static_cast<uint64_t>(g),
+                                    lg->lookahead, lg->regenerate ? 0 : 1, lg->replay_entries);
+}
+
+// the check jobs of slot s; a replay check's expected bytes are the entry its request carried
+void append_checks(const tb200_loadgen* lg, int s, std::vector<tb200_check_job>& out) {
+  const tb200_check_job* first = lg->check_jobs.data() + static_cast<size_t>(s) * lg->check_per_slot;
+  if (lg->check_b_stride.empty()) {  // no replay check: the slot's jobs as they are
+    out.insert(out.end(), first, first + lg->check_per_slot);
+    return;
+  }
+  const int per_image = lg->check_per_slot / static_cast<int>(lg->lookahead);
+  for (int k = 0; k < lg->check_per_slot; ++k) {
+    tb200_check_job job = first[k];
+    if (lg->check_b_stride[static_cast<size_t>(k)] != 0) {
+      job.b += replay_entry_of(lg, s, k / per_image) * lg->check_b_stride[static_cast<size_t>(k)];
+    }
+    out.push_back(job);
+  }
+}
+
+// the copies that write the entries of slot s's current generation into its inputs
+void append_copies(const tb200_loadgen* lg, int s, std::vector<tb200_copy_job>& out) {
+  const int per_image = lg->copy_per_slot / static_cast<int>(lg->lookahead);
+  for (int j = 0; j < lg->copy_per_slot; ++j) {
+    tb200_copy_job job = lg->copy_jobs[static_cast<size_t>(s) * lg->copy_per_slot + j];
+    job.src += replay_entry_of(lg, s, j / per_image) * lg->copy_stride[static_cast<size_t>(j)];
+    out.push_back(job);
+  }
+}
 
 void h2_flush_ctrl(Conn& c);
 
@@ -806,8 +847,10 @@ void device_main_pipelined(tb200_loadgen* lg) {
   std::vector<Pass> pool(depth);  // reused vectors, one per ring position
   uint64_t seq = 0;
   std::vector<tb200_fill_job> fills;
+  std::vector<tb200_copy_job> copies;
   const bool do_check = lg->check_per_slot > 0;
   const bool do_fill = lg->regenerate && lg->fill_per_slot > 0;
+  const bool do_copy = lg->regenerate && lg->replay_entries > 0;
 
   auto retire = [&](Pass& p) {
     uint64_t bad = 0, mism = 0;
@@ -863,9 +906,14 @@ void device_main_pipelined(tb200_loadgen* lg) {
       p.batch.swap(batch);
       p.checks.clear();
       fills.clear();
+      copies.clear();
       if (do_check) {
+        for (int s : p.batch) append_checks(lg, s, p.checks);
+      }
+      if (do_copy) {
         for (int s : p.batch) {
-          for (int k = 0; k < lg->check_per_slot; ++k) p.checks.push_back(lg->check_jobs[s * lg->check_per_slot + k]);
+          lg->replay_gen[static_cast<size_t>(s)] += 1;
+          append_copies(lg, s, copies);
         }
       }
       if (do_fill) {
@@ -876,8 +924,13 @@ void device_main_pipelined(tb200_loadgen* lg) {
       }
       p.results = lg->own_results + (seq % depth) * max_checks;
       p.results_host = static_cast<const tb200_check_result*>(lg->own_results_host) + (seq % depth) * max_checks;
-      p.rc = tb200_step_submit(lg->ctx, fills.data(), static_cast<int>(fills.size()), lg->seed, lg->epoch, p.checks.data(),
-                               static_cast<int>(p.checks.size()), p.results, &p.ticket);
+      if (do_copy) {
+        p.rc = tb200_step_submit_copy(lg->ctx, copies.data(), static_cast<int>(copies.size()), p.checks.data(),
+                                      static_cast<int>(p.checks.size()), p.results, &p.ticket);
+      } else {
+        p.rc = tb200_step_submit(lg->ctx, fills.data(), static_cast<int>(fills.size()), lg->seed, lg->epoch, p.checks.data(),
+                                 static_cast<int>(p.checks.size()), p.results, &p.ticket);
+      }
       ++seq;
       inflight.push_back(std::move(p));
       if (inflight.size() < depth) continue;  // room for another pass: look for returned slots first
@@ -903,6 +956,7 @@ void device_main(tb200_loadgen* lg) {
   std::vector<int> batch;
   std::vector<tb200_fill_job> fills;
   std::vector<tb200_check_job> checks;
+  std::vector<tb200_copy_job> copies;
   while (!lg->stop.load(std::memory_order_relaxed)) {
     batch.clear();
     const int first = lg->returned.pop(50);
@@ -928,11 +982,17 @@ void device_main(tb200_loadgen* lg) {
       uint64_t bad = 0, mism = 0;
       const bool do_check = lg->check_per_slot > 0;
       const bool do_fill = lg->regenerate && lg->fill_per_slot > 0;
+      const bool do_copy = lg->regenerate && lg->replay_entries > 0;
       checks.clear();
       fills.clear();
+      copies.clear();
       if (do_check) {
+        for (int s : batch) append_checks(lg, s, checks);
+      }
+      if (do_copy) {
         for (int s : batch) {
-          for (int k = 0; k < lg->check_per_slot; ++k) checks.push_back(lg->check_jobs[s * lg->check_per_slot + k]);
+          lg->replay_gen[static_cast<size_t>(s)] += 1;
+          append_copies(lg, s, copies);
         }
       }
       if (do_fill) {
@@ -946,7 +1006,11 @@ void device_main(tb200_loadgen* lg) {
       // 1 = check, sync, fill, sync; 2 = one stream, one sync
       static const int mode = getenv("TB200_LOADGEN_DEVICE_MODE") ? atoi(getenv("TB200_LOADGEN_DEVICE_MODE")) : 0;
       int rc = TB200_OK;
-      if (do_fill && mode == 0) {
+      if (do_copy) {  // replayed entries: validate, copy the next entries, one sync
+        if (do_check) rc = tb200_check_async(lg->ctx, checks.data(), static_cast<int>(checks.size()), lg->results);
+        if (rc == TB200_OK) rc = tb200_concat_async(lg->ctx, copies.data(), static_cast<int>(copies.size()));
+        if (rc == TB200_OK) rc = tb200_ctx_sync(lg->ctx);
+      } else if (do_fill && mode == 0) {
         rc = tb200_step_sync(lg->ctx, fills.data(), static_cast<int>(fills.size()), lg->seed, lg->epoch,
                              checks.data(), static_cast<int>(checks.size()), lg->results);
       } else {
@@ -1034,7 +1098,22 @@ int tb200_loadgen_create(const tb200_loadgen_config* cfg, tb200_loadgen** out) {
                                                                       : (lg->grpc_stream ? "/inference.GRPCInferenceService/ModelStreamInfer"
                                                                                          : "/inference.GRPCInferenceService/ModelInfer"));
   }
-  if (cfg->ctx != nullptr && cfg->fill_jobs != nullptr && cfg->fill_jobs_per_slot > 0) {
+  if (cfg->ctx != nullptr && cfg->replay_entries > 0) {
+    const int L = static_cast<int>(lg->lookahead);
+    if (cfg->copy_jobs == nullptr || cfg->copy_jobs_per_slot <= 0 || cfg->copy_src_stride == nullptr ||
+        cfg->copy_jobs_per_slot % L != 0 || (cfg->check_jobs_per_slot > 0 && cfg->check_jobs_per_slot % L != 0)) {
+      delete lg;
+      return lg_fail(TB200_ERR_INVALID, "replayed inputs need copy jobs (and check jobs) for every staging image of a slot");
+    }
+    lg->replay_entries = cfg->replay_entries;
+    lg->copy_per_slot = cfg->copy_jobs_per_slot;
+    lg->copy_jobs.assign(cfg->copy_jobs, cfg->copy_jobs + static_cast<size_t>(cfg->concurrency) * cfg->copy_jobs_per_slot);
+    lg->copy_stride.assign(cfg->copy_src_stride, cfg->copy_src_stride + cfg->copy_jobs_per_slot);
+    if (cfg->check_b_stride != nullptr && cfg->check_jobs_per_slot > 0) {
+      lg->check_b_stride.assign(cfg->check_b_stride, cfg->check_b_stride + cfg->check_jobs_per_slot);
+    }
+    lg->replay_gen.assign(static_cast<size_t>(cfg->concurrency), 0);
+  } else if (cfg->ctx != nullptr && cfg->fill_jobs != nullptr && cfg->fill_jobs_per_slot > 0) {
     lg->fill_per_slot = cfg->fill_jobs_per_slot;
     lg->fill_jobs.assign(cfg->fill_jobs, cfg->fill_jobs + static_cast<size_t>(cfg->concurrency) * cfg->fill_jobs_per_slot);
   }
@@ -1047,7 +1126,7 @@ int tb200_loadgen_create(const tb200_loadgen_config* cfg, tb200_loadgen** out) {
     lg->tails.assign(cfg->tails, cfg->tails + cfg->concurrency);
     lg->tail_sizes.assign(cfg->tail_sizes, cfg->tail_sizes + cfg->concurrency);
   }
-  lg->passthrough = lg->ctx == nullptr || (lg->check_per_slot == 0 && !(lg->regenerate && lg->fill_per_slot > 0));
+  lg->passthrough = lg->ctx == nullptr || (lg->check_per_slot == 0 && !(lg->regenerate && (lg->fill_per_slot > 0 || lg->replay_entries > 0)));
   lg->pipeline_depth = cfg->pipeline_depth == 0 ? 1u : std::min<uint32_t>(cfg->pipeline_depth, TB200_STEP_DEPTH / 2);
   if (getenv("TB200_LOADGEN_DEVICE_MODE") != nullptr) lg->pipeline_depth = 1;  // the experiment modes are synchronous
   if (lg->pipeline_depth > 1 && !lg->passthrough) {
@@ -1066,10 +1145,25 @@ int tb200_loadgen_create(const tb200_loadgen_config* cfg, tb200_loadgen** out) {
   return TB200_OK;
 }
 
+uint64_t tb200_loadgen_replay_entry(uint64_t slot, uint64_t request, uint32_t lookahead, int once, uint64_t entries) {
+  if (entries == 0) return 0;
+  const uint64_t r = once ? request % (lookahead > 1 ? lookahead : 1) : request;
+  return (slot % entries + r % entries) % entries;
+}
+
 int tb200_loadgen_start(tb200_loadgen* lg) {
   if (lg == nullptr || lg->started) return lg_fail(TB200_ERR_STATE, "load generator already started");
   // initial generation of every slot: one launch
-  if (lg->ctx != nullptr && lg->fill_per_slot > 0) {
+  if (lg->ctx != nullptr && lg->replay_entries > 0) {
+    std::vector<tb200_copy_job> copies;
+    for (int s = 0; s < lg->concurrency; ++s) {
+      lg->replay_gen[static_cast<size_t>(s)] = 0;
+      append_copies(lg, s, copies);
+    }
+    if (tb200_concat_async(lg->ctx, copies.data(), static_cast<int>(copies.size())) != 0 || tb200_ctx_sync(lg->ctx) != 0) {
+      return lg_fail(TB200_ERR_CUDA, tb200_last_error());
+    }
+  } else if (lg->ctx != nullptr && lg->fill_per_slot > 0) {
     if (tb200_fill_async(lg->ctx, lg->fill_jobs.data(), static_cast<int>(lg->fill_jobs.size()), lg->seed, 0) != 0 ||
         tb200_ctx_sync(lg->ctx) != 0) {
       return lg_fail(TB200_ERR_CUDA, tb200_last_error());

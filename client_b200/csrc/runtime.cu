@@ -1463,9 +1463,14 @@ int tb200_step_wait(tb200_ctx* ctx, uint64_t ticket) {
   return TB200_OK;
 }
 
-int tb200_step_submit(tb200_ctx* ctx, const tb200_fill_job* fill_jobs, int nfill, uint64_t seed,
-                      uint64_t stream_epoch, const tb200_check_job* check_jobs, int ncheck,
-                      tb200_check_result* results, uint64_t* ticket) {
+// One pipelined step: `write_inputs` issues the input side (a fill, or the copies of replayed
+// entries) on the main stream, the checks go to the side stream, and the ring entry's events
+// follow both.
+extern "C++" {
+namespace {
+template <typename WriteInputs>
+int step_submit_with(tb200_ctx* ctx, WriteInputs&& write_inputs, const tb200_check_job* check_jobs, int ncheck,
+                     tb200_check_result* results, uint64_t* ticket) {
   if (ctx == nullptr || ticket == nullptr) return fail(TB200_ERR_INVALID, "ctx / ticket is NULL");
   if (ctx->forked || ctx->capture != nullptr) return fail(TB200_ERR_STATE, "step inside a fork / capture");
   DeviceGuard g(ctx->device);
@@ -1484,7 +1489,7 @@ int tb200_step_submit(tb200_ctx* ctx, const tb200_fill_job* fill_jobs, int nfill
     TB200_CUDA(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
     TB200_CUDA(cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming));
   }
-  int rc = tb200_fill_async(ctx, fill_jobs, nfill, seed, stream_epoch);
+  int rc = write_inputs();
   if (rc != TB200_OK) return rc;
   TB200_CUDA(cudaEventRecord(ctx->step_ev[k][0], ctx->stream));
   ctx->step_has_side[k] = ncheck > 0;
@@ -1504,6 +1509,20 @@ int tb200_step_submit(tb200_ctx* ctx, const tb200_fill_job* fill_jobs, int nfill
   ctx->step_next = t + 1;
   *ticket = t;
   return TB200_OK;
+}
+}  // namespace
+}  // extern "C++"
+
+int tb200_step_submit(tb200_ctx* ctx, const tb200_fill_job* fill_jobs, int nfill, uint64_t seed,
+                      uint64_t stream_epoch, const tb200_check_job* check_jobs, int ncheck,
+                      tb200_check_result* results, uint64_t* ticket) {
+  return step_submit_with(
+      ctx, [&] { return tb200_fill_async(ctx, fill_jobs, nfill, seed, stream_epoch); }, check_jobs, ncheck, results, ticket);
+}
+
+int tb200_step_submit_copy(tb200_ctx* ctx, const tb200_copy_job* copies, int ncopy, const tb200_check_job* check_jobs,
+                           int ncheck, tb200_check_result* results, uint64_t* ticket) {
+  return step_submit_with(ctx, [&] { return tb200_concat_async(ctx, copies, ncopy); }, check_jobs, ncheck, results, ticket);
 }
 
 int tb200_tune(const char* key, int value) {

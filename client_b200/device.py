@@ -413,6 +413,14 @@ class DeviceOps:
         _native.check(self._lib.tb200_step_submit(self._ctx.handle, fa, nf, seed, epoch, ca, nc, results_ptr, self._ticket_ref))
         return ticket.value
 
+    def step_submit_copy(self, copy_jobs, check_jobs, results_ptr):
+        """step_submit with the inputs copied (tb200_step_submit_copy): the copy jobs run as one
+        concat launch on the main stream, the checks on the side stream.  Returns a ticket for step_wait()."""
+        ca, nc = self.job_array(copy_jobs, CopyJob)
+        ka, nk = self.job_array(check_jobs, CheckJob)
+        _native.check(self._lib.tb200_step_submit_copy(self._ctx.handle, ca, nc, ka, nk, results_ptr, self._ticket_ref))
+        return self._ticket.value
+
     def step_wait(self, ticket):
         """Returns when the step's inputs are generated and its results are visible."""
         _native.check(self._lib.tb200_step_wait(self._ctx.handle, ticket))

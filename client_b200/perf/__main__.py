@@ -1,3 +1,5 @@
-from .cli import main
+import sys
 
-main()
+from .cli import exit_status, main
+
+sys.exit(exit_status(main()))

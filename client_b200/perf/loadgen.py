@@ -23,6 +23,7 @@ import numpy as np
 
 from .. import _native
 from ..utils import InferenceServerException, deserialize_bytes_tensor, triton_to_np_dtype
+from .input_data import InputDataError, replay_entry
 
 
 class TensorSpec:
@@ -65,11 +66,20 @@ class InferStat:
 
 
 class SlotSet:
-    """Per-slot input/output buffers and their device job tables."""
+    """Per-slot input/output buffers and their device job tables.
+
+    ``replay``: an ``input_data.InputData`` (``--input-data FILE|DIR``).  The slots' inputs are
+    then copied from its device pool instead of generated, and outputs named in its
+    ``validation_data`` are compared bytewise with the expected entry (cuda shm only)."""
 
     def __init__(self, inputs, outputs, slots, shared_memory, device_id, input_data, seed, token_range=None,
-                 name_prefix="tb200", staging=None, wire_prefixes=None, lookahead=1):
+                 name_prefix="tb200", staging=None, wire_prefixes=None, lookahead=1, replay=None):
         self.inputs, self.outputs, self.slots = inputs, outputs, slots
+        self.replay = replay
+        if replay is not None and replay.expected and shared_memory != "cuda":
+            raise InputDataError("validation_data is checked on the device, which holds the outputs only with --shared-memory cuda")
+        self._gen = [-1] * slots  # replay: the generation each slot's inputs hold (-1: not written yet)
+        self.validation_mismatches = 0  # bytes that differ from validation_data, over all validate() calls
         # wire mode + native engine: every slot owns `lookahead` staging images that one device
         # pass generates together; the transport sends them one after the other and returns the
         # slot to the device thread only when all are used (every request still carries fresh
@@ -130,6 +140,8 @@ class SlotSet:
                         view[:] = b
         self._results = None
         self._result_view = None
+        if replay is not None and self._staging is None:
+            replay.upload(self._ops)
 
     # -- layout ------------------------------------------------------------------------
     def input_offset(self, slot, index, generation=0):
@@ -171,11 +183,55 @@ class SlotSet:
                                           stream_id=(image << 8) | i, mode=mode, low=lo, high=hi))
         return jobs
 
+    def entry(self, slot, image=0):
+        """The replayed entry that image ``image`` of the slot's current generation carries."""
+        return replay_entry(slot, self._gen[slot] * self.lookahead + image, self.lookahead, False, self.replay.entries)
+
+    def _copy_jobs(self, slot_ids, at_entry=None):
+        """Copies of replayed entries into the inputs of the given slots (slot, image, input order,
+        like _fill_jobs): each image's own entry, or entry ``at_entry`` everywhere."""
+        from .._native import CopyJob
+
+        jobs = []
+        for s, g in ((s, g) for s in slot_ids for g in range(self.lookahead)):
+            e = self.entry(s, g) if at_entry is None else at_entry
+            for i, t in enumerate(self.inputs):
+                jobs.append(CopyJob(dst=self.in_base + self.input_offset(s, i, g), src=self.replay.input_ptr(t.name) + e * t.nbytes, nbytes=t.nbytes))
+        return jobs
+
+    def _check_jobs(self, slot_ids, at_entry=None):
+        """Validation of the outputs of the given slots (slot, image, output order): EQUAL against the
+        replayed entry for outputs named in validation_data, else TOP1 (FP32) / SUM."""
+        from .._native import CheckJob
+
+        expected = self.replay.expected if self.replay is not None else {}
+        jobs = []
+        for s, g in ((s, g) for s in slot_ids for g in range(self.lookahead)):
+            for i, t in enumerate(self.outputs):
+                a = self.out_base + self.output_offset(s, i, g)
+                if t.name in expected:
+                    e = self.entry(s, g) if at_entry is None else at_entry
+                    jobs.append(CheckJob(a=a, b=self.replay.expected_ptr(t.name) + e * t.nbytes, nbytes=t.nbytes, kind=_native.CHECK_EQUAL))
+                else:
+                    jobs.append(CheckJob(a=a, nbytes=t.nbytes, kind=_native.CHECK_TOP1 if t.datatype == "FP32" else _native.CHECK_SUM))
+        return jobs
+
     def generate(self, slot_ids):
-        """(Re)generate the inputs of the given slots: one launch, returns when visible."""
+        """(Re)generate the inputs of the given slots: one launch, returns when visible.  With
+        replayed data every slot moves on to its next generation's entries."""
         if not slot_ids:
             return
-        if self._staging is not None:
+        if self.replay is not None:
+            for s in slot_ids:
+                self._gen[s] += 1
+            if self._staging is not None:
+                for s, g in ((s, g) for s in slot_ids for g in range(self.lookahead)):
+                    for i, t in enumerate(self.inputs):
+                        self._staging.view(self.input_offset(s, i, g), t.nbytes)[:] = self.replay.inputs[t.name][self.entry(s, g)]
+            else:
+                self._ops.concat(self._copy_jobs(slot_ids))
+                self._ops.sync()
+        elif self._staging is not None:
             self._staging.fill([(self.input_offset(s, i, g), t) for s in slot_ids for g in range(self.lookahead) for i, t in enumerate(self.inputs)],
                                self.input_data, self.seed + self.epoch)
         else:
@@ -195,27 +251,26 @@ class SlotSet:
         return self._wire.view(off, self.in_bytes)
 
     def validate(self, slot_ids):
-        """Device-side checksum / top-1 of the outputs of the given slots (cuda shm);
-        returns the number of non-finite values seen (0 expected)."""
+        """Device-side checksum / top-1 of the outputs of the given slots (cuda shm), and the
+        bytewise comparison with validation_data (added to ``validation_mismatches``); returns the
+        number of non-finite values seen (0 expected)."""
         if self.shared_memory != "cuda" or not slot_ids or not self.outputs:
             return 0
-        from .._native import CheckJob
         from ..device import HostBuffer, results_array
 
         if self._results is None:
-            self._results = HostBuffer(self.slots * len(self.outputs) * 32)
-            self._result_view = results_array(self._results, self.slots * len(self.outputs))
-        jobs = []
-        for s in slot_ids:
-            for i, t in enumerate(self.outputs):
-                kind = _native.CHECK_TOP1 if t.datatype == "FP32" else _native.CHECK_SUM
-                jobs.append(CheckJob(a=self.out_base + self.output_offset(s, i), nbytes=t.nbytes, kind=kind))
+            n = self.slots * self.lookahead * len(self.outputs)
+            self._results = HostBuffer(n * 32)
+            self._result_view = results_array(self._results, n)
+        jobs = self._check_jobs(slot_ids)
         self._ops.check(jobs, self._results.device_ptr)
         self._ops.sync()
         bad = 0
         for k, job in enumerate(jobs):
             if job.kind == _native.CHECK_TOP1:
                 bad += int(self._result_view["mismatches"][k])
+            elif job.kind == _native.CHECK_EQUAL:
+                self.validation_mismatches += int(self._result_view["mismatches"][k])
         return bad
 
     # -- server registration --------------------------------------------------------------------
@@ -422,11 +477,14 @@ def measure(manager, interval_ms=1000, stability_pct=10.0, max_trials=10, percen
     within ``stability_pct`` in throughput and latency, or ``max_trials`` windows."""
     manager.swap_records()
     windows = []
+    seen = manager.slotset.validation_mismatches
     for _ in range(max_trials):
         t0 = time.perf_counter()
         time.sleep(interval_ms / 1e3)
         recs = manager.swap_records()
         windows.append(summarize(recs, time.perf_counter() - t0, percentile))
+        now = manager.slotset.validation_mismatches
+        windows[-1]["validation_mismatches"], seen = now - seen, now
         if len(windows) >= min_windows:
             last = windows[-min_windows:]
             thr = [w["throughput"] for w in last]
@@ -441,4 +499,5 @@ def measure(manager, interval_ms=1000, stability_pct=10.0, max_trials=10, percen
     merged["windows"] = len(windows)
     merged["stable"] = len(windows) < max_trials or len(windows) == min_windows
     merged["count"] = total
+    merged["validation_mismatches"] = sum(w["validation_mismatches"] for w in last)
     return merged

@@ -100,24 +100,31 @@ class NativeLoadGenerator:
             cfg.tail_sizes = (ctypes.c_uint64 * n)(*[s for _, s in tails])
         if ss._ops is not None:
             cfg.ctx = ss._ops.ctx.handle
-            fills = ss._fill_jobs(list(range(n)))
             per = len(ss.inputs) * ss.lookahead
-            cfg.fill_jobs = (_native.FillJob * len(fills))(*fills)
-            cfg.fill_jobs_per_slot = per
+            if ss.replay is not None:
+                # replayed entries: templates at entry 0, the device thread adds entry * tensor size
+                copies = ss._copy_jobs(list(range(n)), at_entry=0)
+                cfg.replay_entries = ss.replay.entries
+                cfg.copy_jobs = (_native.CopyJob * len(copies))(*copies)
+                cfg.copy_jobs_per_slot = per
+                cfg.copy_src_stride = (ctypes.c_uint64 * per)(*[t.nbytes for _ in range(ss.lookahead) for t in ss.inputs])
+            else:
+                fills = ss._fill_jobs(list(range(n)))
+                cfg.fill_jobs = (_native.FillJob * len(fills))(*fills)
+                cfg.fill_jobs_per_slot = per
             cfg.seed = ss.seed
             cfg.regenerate = 1 if regenerate else 0
             if validate and ss.shared_memory == "cuda" and ss.outputs:
                 from ..device import HostBuffer
 
-                checks = []
-                for s, g in ((s, g) for s in range(n) for g in range(ss.lookahead)):
-                    for i, t in enumerate(ss.outputs):
-                        kind = _native.CHECK_TOP1 if t.datatype == "FP32" else _native.CHECK_SUM
-                        checks.append(_native.CheckJob(a=ss.out_base + ss.output_offset(s, i, g), nbytes=t.nbytes, kind=kind))
+                checks = ss._check_jobs(list(range(n)), at_entry=0)
                 self._results = HostBuffer(len(checks) * 32)
                 cfg.check_jobs = (_native.CheckJob * len(checks))(*checks)
                 cfg.check_jobs_per_slot = len(ss.outputs) * ss.lookahead
                 cfg.results = self._results.device_ptr
+                if ss.replay is not None:
+                    strides = [t.nbytes if t.name in ss.replay.expected else 0 for _ in range(ss.lookahead) for t in ss.outputs]
+                    cfg.check_b_stride = (ctypes.c_uint64 * len(strides))(*strides)
         cfg.device_window_us = int(device_window_us)
         cfg.lookahead = ss.lookahead
         cfg.tail_stride = ss.wire_stride

@@ -402,6 +402,13 @@ int tb200_step_submit(tb200_ctx* ctx, const tb200_fill_job* fill_jobs, int nfill
                       uint64_t stream_epoch, const tb200_check_job* check_jobs, int ncheck,
                       tb200_check_result* results, uint64_t* ticket);
 int tb200_step_wait(tb200_ctx* ctx, uint64_t ticket);
+/* The same step with the inputs copied instead of generated: the `ncopy` copy jobs run as one
+ * tb200_concat_async on the context's stream (user-supplied entries replayed from a device-resident
+ * pool, perf --input-data FILE|DIR), the checks on the side stream.  Shares the ticket ring:
+ * tb200_step_wait retires it. */
+int tb200_step_submit_copy(tb200_ctx* ctx, const tb200_copy_job* copies, int ncopy,
+                           const tb200_check_job* check_jobs, int ncheck,
+                           tb200_check_result* results, uint64_t* ticket);
 
 /* knobs: "fill_variant" (experiment matrix of scripts/fill_sweep.py, 0 = default policy);
  * "step_parallel_min_mb": tb200_step_sync runs check and fill as parallel branches only

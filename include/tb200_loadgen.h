@@ -82,7 +82,26 @@ typedef struct tb200_loadgen_config {
    * while the device runs the previous ones, consecutive generations overlap on the device, and
    * slots go back to their connections in pass order.  At most TB200_STEP_DEPTH / 2. */
   uint32_t pipeline_depth;
+  /* replayed inputs (perf --input-data FILE|DIR).  0 entries = off: the fill jobs generate the inputs.
+   * Otherwise `replay_entries` user-supplied entries sit in a device pool and every device pass copies
+   * the next entry of each returned slot into its inputs (tb200_concat_async / tb200_step_submit_copy):
+   * copy_jobs[concurrency * copy_jobs_per_slot] are laid out like fill_jobs (slot-major, then staging
+   * image, then input) and point at entry 0; job j of a slot reads entry e at
+   * src + e * copy_src_stride[j].  check_b_stride[k] (one per check job of a slot) does the same for
+   * the expected bytes `b` of an EQUAL check; 0 leaves check k as it is.  Request r of slot s carries
+   * entry tb200_loadgen_replay_entry(s, r, lookahead, !regenerate, replay_entries), and its response is
+   * checked against the same entry. */
+  uint64_t replay_entries;
+  const tb200_copy_job* copy_jobs;
+  int copy_jobs_per_slot;
+  const uint64_t* copy_src_stride;  /* [copy_jobs_per_slot] */
+  const uint64_t* check_b_stride;   /* [check_jobs_per_slot], may be NULL */
 } tb200_loadgen_config;
+
+/* The entry rule of replayed inputs: (slot + r) mod entries, r = request mod lookahead when the
+ * inputs are written once (`once` != 0, i.e. regenerate == 0); request r of a slot is image g of its
+ * generation k when r = k * lookahead + g. */
+uint64_t tb200_loadgen_replay_entry(uint64_t slot, uint64_t request, uint32_t lookahead, int once, uint64_t entries);
 
 typedef struct tb200_loadgen_stats {
   /* InferStat (reference common.h:93-114) over the window */
